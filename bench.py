@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — CSR SpMV throughput (BASELINE.json metric) on B200, one process per GPU.
+"""bench.py — CSR SpMV throughput (BASELINE.json metric) on H100, one process per GPU.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 \
            --master-port P bench.py --gpus N --steps K --warmup W
 
@@ -13,7 +13,7 @@ regenerates the identical matrix with the generator's host twin in oracle/.
 
 One JSON line is printed by rank 0.  Keys beyond the base contract:
   roofline      HBM roofline of the SpMV launch sequence (pipe kernel + its fix-up kernel, once per
-                column block: the library splits this matrix into 2 column blocks so that the
+                column block: the library splits this matrix into column blocks so that the
                 gathered slice of x stays L2 resident); achieved = plain-CSR algorithmic bytes / time
   e2e           the same metric through the public API with HOST vectors (pinned): N=1
                 csr_array.dot(x_host, out=y_host) — 2-D blocked H2D / compute / D2H pipeline; N>1
@@ -30,6 +30,11 @@ One JSON line is printed by rank 0.  Keys beyond the base contract:
   gathered      (N>1) the variant that all-gathers y (what the public A @ x returns)
   cusparse      (N=1, informative) cuSPARSE SpMV through torch.sparse on the same arrays —
                 the vendor call the reference wraps (spmv.cu:117-152); bench-only
+
+--dump-outputs DIR writes, after the timed steps, the y of the last timed step as DIR/y.npy (fp64;
+DIR/y_rank<r>.npy per rank at N>1) at a fixed, seeded sample of rows when y exceeds the budget,
+with the sampled row ids in DIR/y_rows.npy (y_rows_rank<r>.npy).  Inputs depend on the arguments
+only (seeded generators), so two builds can be compared output for output.
 """
 import argparse
 import json
@@ -62,7 +67,36 @@ def parse():
     ap.add_argument("--no-extras", action="store_true", help="skip the banded / cg / spgemm / powerlaw / cusparse / cpu legs")
     ap.add_argument("--spgemm-scale", type=int, default=0, help="R-MAT scale of the SpGEMM leg (0 = 18 at N=1, 20 at N>=4)")
     ap.add_argument("--pl-rows", type=int, default=8_000_000)
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's y (sampled when large) as DIR/*.npy")
+    args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be >= 1 and --warmup >= 0")
+    return args
+
+
+DUMP_BUDGET = 24 << 20     # bytes of y (+ as many of row ids) per dump, all ranks together: < 64 MB in all
+
+
+def dump_rows(nloc, ranks):
+    """Row ids (local) written by --dump-outputs: all rows when they fit the budget, else a fixed
+    seeded sample, sorted."""
+    cap = DUMP_BUDGET // 8 // ranks
+    if nloc <= cap:
+        return None
+    return np.sort(np.random.default_rng(SEED).choice(nloc, size=cap, replace=False))
+
+
+def dump_outputs(out_dir, y, row0, ranks, rank):
+    """y (host or device, fp64) of the timed path → out_dir/y[_rank<r>].npy (+ global row ids when sampled)."""
+    os.makedirs(out_dir, exist_ok=True)
+    y = y.cpu().numpy() if hasattr(y, "cpu") else np.asarray(y)
+    sel = dump_rows(len(y), ranks)
+    tag = "" if ranks == 1 else f"_rank{rank}"
+    if sel is not None:
+        np.save(os.path.join(out_dir, f"y_rows{tag}.npy"), (sel + row0).astype(np.float64))
+        y = y[sel]
+    np.save(os.path.join(out_dir, f"y{tag}.npy"), np.ascontiguousarray(y, dtype=np.float64))
 
 
 def workload_name(args):
@@ -141,6 +175,17 @@ class Clocks:
 
 
 # ------------------------------------------------------------------ measurement helpers
+def power_limit_w(props):
+    """The card's power limit (W) as nvidia-smi reports it, or None: a number is stated with it."""
+    try:
+        out = subprocess.run(["nvidia-smi", "-i", f"GPU-{props.uuid}",
+                              "--query-gpu=power.limit", "--format=csv,noheader,nounits"],
+                             capture_output=True, text=True, timeout=20)
+        return float(out.stdout.strip().splitlines()[0])
+    except Exception:
+        return None
+
+
 def spmv_bytes(nnz, nrows, ncols, idx_bytes):
     """Algorithmic bytes of one SpMV (SURVEY §8d): every array once."""
     return nnz * (8 + idx_bytes) + (nrows + 1) * 8 + ncols * 8 + nrows * 8
@@ -173,21 +218,15 @@ def timed_steps(fn, steps, warmup, dist_mod):
     return float(total.item()), per
 
 
+HBM_SPEC_GBS = 3350.0   # H100 SXM data sheet (HBM3, 700 W card)
+
+
 def peaks():
     try:
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
-
-
-def known_traffic(tag):
-    """dram bytes/launch from the committed ncu --set full capture (profiles/), or None."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "spmv_traffic.json")) as f:
-            return json.load(f).get(tag)
-    except Exception:
-        return None
+        return HBM_SPEC_GBS, "H100 SXM data sheet (3.35 TB/s); not reached in practice"
 
 
 # ------------------------------------------------------------------ CPU side (oracle port of the reference)
@@ -200,10 +239,12 @@ def host_threads():
         return os.cpu_count() or 1
 
 
-def cpu_spmv_full(n, k, budget_s, warm=1, x=None):
+def cpu_spmv_full(n, k, steps, warmup, x=None):
     """The reference's OpenMP task body (spmv_omp.cc:36-44, oracle/ref_kernels.c) on the FULL bench
     matrix regenerated by the host twin of legate_sparse.random (same seed → same matrix; arrays
-    first-touched by the threads that use them).  Best over {all threads, half}."""
+    first-touched by the threads that use them).  One probe pass each on all host threads and on
+    half of them picks the thread count (SMT siblings can slow it down); then `warmup` passes and
+    exactly `steps` timed passes at that count; y is the last timed pass's result."""
     from oracle import oracle
 
     threads_all = host_threads()
@@ -213,20 +254,22 @@ def cpu_spmv_full(n, k, budget_s, warm=1, x=None):
     if x is None:
         x = oracle.fill_uniform(n, 1)
     gen_s = time.perf_counter() - t0
-    best, y = None, None
-    for threads in sorted({threads_all, max(1, threads_all // 2)}, reverse=True):
-        oracle.omp_set_threads(threads)
-        for _ in range(warm):
-            y = oracle.spmv(indptr, cols, vals, x, omp=True)
-        reps, t1 = 0, time.perf_counter()
-        while reps < 3 or (time.perf_counter() - t1 < budget_s / 2 and reps < 200):
-            y = oracle.spmv(indptr, cols, vals, x, omp=True)
-            reps += 1
-        dt = (time.perf_counter() - t1) / reps
-        if best is None or dt < best[0]:
-            best = (dt, threads, reps)
-    dt, threads, reps = best
-    info = {"seconds_per_spmv": dt, "threads": threads, "reps": reps, "generate_s": gen_s,
+    probe = {}
+    for t in sorted({threads_all, max(1, threads_all // 2)}, reverse=True):
+        oracle.omp_set_threads(t)
+        t1 = time.perf_counter()
+        oracle.spmv(indptr, cols, vals, x, omp=True)
+        probe[t] = time.perf_counter() - t1
+    threads = min(probe, key=probe.get)
+    oracle.omp_set_threads(threads)
+    for _ in range(warmup):
+        oracle.spmv(indptr, cols, vals, x, omp=True)
+    t1 = time.perf_counter()
+    for _ in range(steps):
+        y = oracle.spmv(indptr, cols, vals, x, omp=True)
+    dt = (time.perf_counter() - t1) / steps
+    info = {"seconds_per_spmv": dt, "threads": threads, "steps": steps, "warmup": warmup, "generate_s": gen_s,
+            "thread_probe_s": {str(t): v for t, v in probe.items()},
             "host_cpus": os.cpu_count(), "threads_available": threads_all}
     return info, (indptr, cols, vals, x, y)
 
@@ -239,11 +282,13 @@ def run_reference(args):
     if rank != 0:
         return
     k, n = args.nnz_per_row, args.rows
-    info, _ = cpu_spmv_full(n, k, budget_s=max(4.0, 0.5 * args.steps), warm=max(1, min(args.warmup, 3)))
+    info, (_, _, _, _, y) = cpu_spmv_full(n, k, args.steps, args.warmup)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, y, 0, 1, 0)
     dt = info["seconds_per_spmv"]
     gflops = 2.0 * n * k / dt / 1e9
     sample = (f"the full {n}x{n} matrix ({n * k} nnz) per step, int64 column ids, identical to the GPU arm's matrix "
-              f"(host twin of legate_sparse.random, seed {SEED}); {info['reps']} timed passes")
+              f"(host twin of legate_sparse.random, seed {SEED}); {info['steps']} timed passes on {info['threads']} threads")
     line = {
         "impl": "reference", "metric": METRIC, "value": gflops, "unit": UNIT, "n_gpus": args.gpus,
         "steps": args.steps, "warmup": args.warmup, "ms_per_step": dt * 1e3, "higher_is_better": True,
@@ -305,6 +350,8 @@ def run_b200(args):
     clocks.start()
     launches0 = _native.launch_count()
     total_ms, per = timed_steps(lambda: A.dot_local(x, out=y_loc), args.steps, args.warmup, dist)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, y_loc, r0, G, rank)
     # the counter spans warm-up + timed calls (same launches per call): keep the timed share
     launches = (_native.launch_count() - launches0) * args.steps // (args.steps + args.warmup)
     ms_per_step = total_ms / args.steps
@@ -317,20 +364,11 @@ def run_b200(args):
     peak, peak_src = peaks()
     achieved = B_local / (kernel_ms * 1e-3) / 1e9
     nbk = plan_info["colblock"]["nblocks"] if "colblock" in plan_info else 1   # pipe-kernel launches per step
-    req_ceiling = None
-    if nbk > 1:
-        # the dominant kernel's own ceiling: one L2 request per clock per SM (l1tex→xbar port, ncu:
-        # l1tex__m_l1tex2xbar_req_cycles_active 90 %): gathers + 128-byte stream requests
-        reqs = nnz_loc + (nnz_loc * 12) / 128.0
-        req_ceiling = {"requests_per_step": reqs, "ceiling_ms": reqs / (148 * 1.965e9) * 1e3,
-                       "frac_of_ceiling": reqs / (148 * 1.965e9) * 1e3 / kernel_ms,
-                       "evidence": "profiles/r2_gather_paths.txt, profiles/r2_ncu_spmv_pipe.md"}
+    props = torch.cuda.get_device_properties(dev)
     roofline = {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                "traffic": known_traffic(f"random_n{n}_k{k}_g{G}" + (f"_cb{nbk}" if nbk > 1 else "")),
                 "launches_per_step": nbk, "algorithmic_bytes_per_launch": B_local / nbk, "idx_bytes": 4,
                 "kernel_ms": kernel_ms / nbk,
-                "peak_source": peak_src, "frac_of_8000_spec": achieved / 8000.0,
-                "l2_request_ceiling": req_ceiling,
+                "peak_source": peak_src, "frac_of_datasheet": achieved / HBM_SPEC_GBS,
                 "timed": "the launch sequence of one SpMV call, CUDA events per step: spmv_pipe_kernel + "
                          "spmv_fixup_kernel, once per column block when the operand is column-blocked "
                          "(achieved counts the plain-CSR algorithmic bytes once, not the extra indptr/y passes)"}
@@ -358,15 +396,16 @@ def run_b200(args):
         path = ("csr_array.dot_local(x_pinned_host, out=y_block_pinned_host): every rank uploads 1/N of x, NCCL "
                 "all-gather of x over NVLink, SpMV of its row block, D2H of its rows of y (y row-sharded on the hosts "
                 "like the headline); bytes are per rank")
-    e2e_steps = max(3, min(args.steps, 10))
-    e2e_step()
-    e2e_ms, _ = timed_steps(e2e_step, e2e_steps, 3, dist)
+    e2e_steps = args.steps
+    e2e_step()   # first use builds the 2-D blocks of the host-vector pipeline (one-time set-up)
+    e2e_ms, _ = timed_steps(e2e_step, e2e_steps, args.warmup, dist)
     torch.cuda.synchronize()
     # e2e parity: the host result equals the device-resident result
     e2e_err = float((y_host.to(dev) - y_loc).abs().max().item())
     e2e_val = 2.0 * nnz_total / (e2e_ms / e2e_steps * 1e-3) / 1e9
     e2e = {"value": e2e_val, "unit": UNIT, "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h,
-           "ms_per_step": e2e_ms / e2e_steps, "max_abs_diff_vs_device_path": e2e_err, "path": path}
+           "ms_per_step": e2e_ms / e2e_steps, "steps": e2e_steps, "warmup": args.warmup,
+           "max_abs_diff_vs_device_path": e2e_err, "path": path}
 
     colblock_cfg = None
     if "colblock" in plan_info:
@@ -381,10 +420,11 @@ def run_b200(args):
         "config": {"workload": workload_name(args), "rows": n, "nnz": nnz_total, "index_dtype": "int32",
                    "generator": f"legate_sparse.random(n, n, density={k}/n, rng={SEED}) — counter-based, on the device",
                    "partition": f"1-D row blocks over {G} rank(s), x replicated, y row-sharded",
-                   "l2": "per-step inputs (%.2f GB/rank) exceed the 126 MB L2; no flush between steps"
-                         % (B_local / 1e9),
+                   "l2": "per-step inputs (%.2f GB/rank) exceed the %d MB L2; no flush between steps"
+                         % (B_local / 1e9, props.L2_cache_size >> 20),
                    "plan": plan_info, "colblock": colblock_cfg},
         "effective_hbm_gbs": G * achieved if G == 1 else None,
+        "device": {"name": props.name, "sms": props.multi_processor_count, "power_limit_w": power_limit_w(props)},
         "clocks": None, "e2e": e2e, "gpu_launches": int(launches) * G, "roofline": roofline, "parity": parity,
     }
 
@@ -637,17 +677,17 @@ def powerlaw_leg(args, dist, dev, rank, peak):
     if G == 1:
         try:
             At = torch.sparse_csr_tensor(ptr.to(torch.int32), cols, vals, size=(n, n))
-            for _ in range(3):
+            for _ in range(args.warmup):
                 At @ x
             torch.cuda.synchronize()
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
-            for _ in range(10):
+            for _ in range(args.steps):
                 At @ x
             e1.record()
             torch.cuda.synchronize()
-            cms = e0.elapsed_time(e1) / 10
-            out["cusparse"] = {"ms_per_step": cms, "value": 2.0 * nnz / cms / 1e6, "unit": UNIT,
+            cms = e0.elapsed_time(e1) / args.steps
+            out["cusparse"] = {"ms_per_step": cms, "value": 2.0 * nnz / cms / 1e6, "unit": UNIT, "steps": args.steps,
                                "what": "cusparseSpMV via torch.sparse_csr_tensor @ x, incl. y allocation"}
         except Exception as e:
             out["cusparse"] = {"unavailable": str(e)[:160]}
@@ -673,8 +713,7 @@ def spgemm_leg(args, dist, dev, rank):
     if G > 2:
         # R-MAT rows are skewed: equal-row blocks leave 2/3 of C on rank 0 (at scale 20 that is what has to fit).
         # Balance the intermediate products per rank instead (rows weighted by sum_k nnz(B_k)).  At 2 ranks the
-        # equal-row split is kept: measured 136 ms vs 232 ms product-balanced (profiles/r2_bench_n2.json before /
-        # after) — the heavy rows of the dense-accumulator class, not the products, set the time there.
+        # equal-row split is kept: the heavy rows of the dense-accumulator class, not the products, set the time there.
         row_nnzB = (ptr[1:] - ptr[:-1]).to(torch.float64)
         w = torch.zeros(n, dtype=torch.float64, device=dev)
         rows = torch.repeat_interleave(torch.arange(n, device=dev), (ptr[1:] - ptr[:-1]))
@@ -683,10 +722,12 @@ def spgemm_leg(args, dist, dev, rank):
         partition = f"A row-blocked over {G} rank(s), rows weighted by their intermediate products, B replicated"
         del w, rows, row_nnzB
     try:
-        C = A @ A   # warm-up (allocations)
+        for _ in range(args.warmup):
+            C = None
+            C = A @ A   # warm-up (allocations)
         C = None
         torch.cuda.synchronize()
-        reps = 3
+        reps = args.steps
         if G > 1:
             import torch.distributed as td
 
@@ -712,8 +753,8 @@ def spgemm_leg(args, dist, dev, rank):
         check = spgemm_row_check(data, idx, ptr, n, blk)
         low = ((2 * nnzA + nnzC) * 12 + 3 * (n + 1) * 8)
         out = {"workload": f"R-MAT scale {scale} (n={n}, nnz(A)={nnzA}): C = A @ A, fp64, int32 column ids",
-               "scale": scale, "why_not_scale_22": "nnz(C) ~ 80 G entries (~1 TB) exceeds 8 x 180 GB; largest fitting scale used",
-               "ms": ms, "products": prod, "products_per_s": prod / (ms * 1e-3), "gflops": 2.0 * prod / ms / 1e6,
+               "scale": scale, "why_not_scale_22": "nnz(C) ~ 80 G entries (~1 TB) exceeds 8 x 80 GB; largest fitting scale used",
+               "ms": ms, "steps": reps, "products": prod, "products_per_s": prod / (ms * 1e-3), "gflops": 2.0 * prod / ms / 1e6,
                "nnzC": nnzC, "compression": prod / max(nnzC, 1),
                "lower_bound_bytes": low, "lower_bound_gbs": low / ms / 1e6,
                "partition": partition + ", C row-sharded (per-rank nnz all-gathered only)",
@@ -766,11 +807,11 @@ def cusparse_leg(vals, cols, indptr, x, n, args):
 
     try:
         At = torch.sparse_csr_tensor(indptr.to(torch.int32), cols, vals, size=(n, n))
-        for _ in range(3):
+        for _ in range(args.warmup):
             yt = At @ x
         torch.cuda.synchronize()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        steps = max(3, min(args.steps, 10))
+        steps = args.steps
         e0.record()
         for _ in range(steps):
             yt = At @ x
@@ -778,19 +819,19 @@ def cusparse_leg(vals, cols, indptr, x, n, args):
         torch.cuda.synchronize()
         ms = e0.elapsed_time(e1) / steps
         del yt
-        return {"value": 2.0 * vals.numel() / (ms * 1e-3) / 1e9, "unit": UNIT, "ms_per_step": ms,
+        return {"value": 2.0 * vals.numel() / (ms * 1e-3) / 1e9, "unit": UNIT, "ms_per_step": ms, "steps": steps,
                 "what": "cusparseSpMV via torch.sparse_csr_tensor @ x (int32 indices), includes y allocation"}
     except Exception as e:  # informative leg only
         return {"unavailable": str(e)[:200]}
 
 
 def cpu_baseline_leg(args, y_gpu, x_np):
-    """Oracle port of the reference's OpenMP task on the host cores, FULL matrix (about 10-20 s incl.
-    generating it), and the GPU's y checked against the CPU's y on ALL rows."""
+    """Oracle port of the reference's OpenMP task on the host cores, FULL matrix, --warmup + --steps
+    passes, and the GPU's y checked against the CPU's y on ALL rows."""
     import scipy.sparse as sp
 
     k, n = args.nnz_per_row, args.rows
-    info, (indptr, cols, vals, x, y_cpu) = cpu_spmv_full(n, k, budget_s=8.0, x=np.ascontiguousarray(x_np))
+    info, (indptr, cols, vals, x, y_cpu) = cpu_spmv_full(n, k, args.steps, args.warmup, x=np.ascontiguousarray(x_np))
     dt = info["seconds_per_spmv"]
     yg = y_gpu.cpu().numpy()
     err = float(np.linalg.norm(yg - y_cpu) / np.linalg.norm(y_cpu))
@@ -798,13 +839,15 @@ def cpu_baseline_leg(args, y_gpu, x_np):
     rows_s = min(n, 1_000_000)
     S = sp.csr_array((vals[: rows_s * k], cols[: rows_s * k].astype(np.int32), indptr[: rows_s + 1].astype(np.int32)),
                      shape=(rows_s, n))
-    S @ x
-    t1 = time.perf_counter()
-    for _ in range(3):
+    for _ in range(args.warmup):
         S @ x
-    dts = (time.perf_counter() - t1) / 3
+    t1 = time.perf_counter()
+    for _ in range(args.steps):
+        S @ x
+    dts = (time.perf_counter() - t1) / args.steps
     return {"value": 2.0 * n * k / dt / 1e9, "unit": UNIT, "cores": info["threads"], "kind": "port",
-            "sample": f"the full {n}x{n} matrix ({n * k} nnz), {info['reps']} passes of the OpenMP SpMV "
+            "steps": args.steps, "warmup": args.warmup,
+            "sample": f"the full {n}x{n} matrix ({n * k} nnz), {info['steps']} passes of the OpenMP SpMV "
                       f"(oracle restatement of spmv_omp.cc:36-44), matrix regenerated on the host in {info['generate_s']:.1f} s",
             "full_y_relerr_gpu_vs_cpu": err, "rows_compared": n, "tolerance": 1e-10,
             "scipy_single_thread_gflops": 2.0 * rows_s * k / dts / 1e9,

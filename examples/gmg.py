@@ -7,7 +7,7 @@ reference's examples/gmg.py (BASELINE config 3), written against this repo's leg
   * weighted-Jacobi smoother from A.diagonal();
   * one V-cycle per CG iteration, handed to linalg.cg as a LinearOperator preconditioner.
 
-All vectors are CUDA tensors, so every A @ x inside the cycle is the sm_100a SpMV and the
+All vectors are CUDA tensors, so every A @ x inside the cycle is the sm_90a SpMV and the
 element-wise smoother arithmetic stays on the device.
 
     python examples/gmg.py -n 512 -l 4

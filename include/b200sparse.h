@@ -1,5 +1,5 @@
 /*
- * b200sparse.h — C ABI of libb200sparse.so, the B200 (sm_100a) sparse hot path.
+ * b200sparse.h — C ABI of libb200sparse.so, the H100 (sm_90a) sparse hot path.
  *
  * This header is the drop-in boundary (SURVEY.md §8b).  The reference
  * (nv-legate/legate-sparse @ 49271fa) exports exactly one C symbol,

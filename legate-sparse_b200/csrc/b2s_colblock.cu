@@ -1,14 +1,14 @@
 // b2s_colblock.cu — column-blocked copy of a CSR matrix for SpMV with an x vector that does not
 // stay resident in L2.
 //
-// Measured on B200 (profiles/README.md, "x residency"): with 10M x 10M / 50 nnz per row fp64 the
-// gathers of x (80 MB) hit L2 only ~43% of the time and the kernel is bound by the L2/DRAM gather
-// rate (3.0 ms); the same non-zeros against a 40 MB x run at 1.16-1.25 ms per 250M nnz.  So the
-// matrix is split once into `nblocks` column blocks A = [A_0 | A_1 | ...] (each a self-contained
-// CSR with global column ids, stable within a row) and y = A x is evaluated as
+// An x that does not stay resident in L2 next to the streamed matrix turns every gather into a
+// DRAM access.  So the matrix is split once into `nblocks` column blocks A = [A_0 | A_1 | ...]
+// (each a self-contained CSR with global column ids, stable within a row) and y = A x is evaluated as
 //     y  = A_0 x ;  y += A_1 x ; ...
 // by the same TMA pipe kernel (accumulate flag), one launch per block, so that every launch
-// gathers from one <= ~40 MB slice of x.  Extra traffic: one more pass over indptr and y per block.
+// gathers from one <= ~20 MB slice of x.  Extra traffic: one more pass over indptr and y per block.
+// Measured on an H100 SXM (50 MB L2, 700 W), 10M x 10M / 50 nnz per row fp64 (x = 80 MB), ms per
+// SpMV: 40 MB slices (2 blocks) 8.60, 27 MB (3) 5.64, 20 MB (4) 4.89, 13 MB (6) 4.86.
 //
 // Replaces nothing in the reference by itself: it is a plan-time layout of the operand of
 // legate_sparse's CSR SpMV task body (src/sparse/array/csr/spmv.cu:30-163): the reference hands the
@@ -127,8 +127,8 @@ __global__ void colblock_sample_kernel(int64_t nrows, const int64_t* __restrict_
 
 static int64_t block_bytes_target() {
   const char* e = getenv("B2S_COLBLOCK_MB");
-  int64_t mb = e ? atoll(e) : 40;
-  if (mb < 1) mb = 40;
+  int64_t mb = e ? atoll(e) : 20;
+  if (mb < 1) mb = 20;
   return mb << 20;
 }
 
@@ -286,7 +286,7 @@ extern "C" int b2s_csr_colblock_create(b2s_dtype vt, b2s_itype it, int64_t nrows
     if (e != cudaSuccess) { delete C; set_error("colblock scatter failed: %s", cudaGetErrorString(e)); return B2S_ERR_CUDA; }
   }
   // one SpMV plan per block, 1024-nnz tiles: the two ping-pong consumer groups of the pipe kernel
-  // measured fastest with them (2.23 ms vs 2.47 ms with 2048-nnz tiles on C2, profiles/r2_pipe_sweep.txt)
+  // measured fastest with them (against 2048-nnz tiles on C2)
   for (int b = 0; b < nb && rc == B2S_OK; ++b) {
     if (C->blk_nnz[b] == 0) continue;
     const int64_t wsb = b2s_spmv_plan_workspace_bytes(nrows, C->blk_nnz[b]);

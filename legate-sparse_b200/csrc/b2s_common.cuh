@@ -1,4 +1,4 @@
-// b2s_common.cuh — shared device/host helpers for libb200sparse (sm_100a only).
+// b2s_common.cuh — shared device/host helpers for libb200sparse (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>
@@ -44,7 +44,7 @@ extern std::atomic<int64_t> g_launch_count;
     }                                                                                \
   } while (0)
 
-constexpr int kNumSMs = 148;  // B200: 2 dies x 74 SMs
+constexpr int kNumSMs = 132;  // H100 SXM
 
 // ---------------------------------------------------------------- value types
 struct c64  { float re, im; };
@@ -238,8 +238,8 @@ template <> __device__ __forceinline__ c128 ld_gather<c128>(const c128* p, uint6
   return r;
 }
 
-// the same without allocating an L1 line: the gathers of the products consumer hit L1 0.5 % of the
-// time, and an L1 line per outstanding request only shrinks what the miss path can keep in flight
+// the same without allocating an L1 line: the random gathers of the products consumer almost never
+// hit L1, and an L1 line per outstanding request only shrinks what the miss path can keep in flight
 template <typename T> __device__ __forceinline__ T ld_gather_na(const T* p, uint64_t pol);
 template <> __device__ __forceinline__ float ld_gather_na<float>(const float* p, uint64_t pol) {
   float r;

@@ -14,7 +14,7 @@
 namespace b2s {
 
 constexpr int kGmThreads   = 256;
-constexpr int kGmMaxBlocks = kNumSMs * 8;   // 1184, like the other reductions
+constexpr int kGmMaxBlocks = kNumSMs * 8;   // like the other reductions
 constexpr int kGmMaxK      = 1024;          // basis vectors per update launch (h staged in shared memory)
 
 template <typename V> struct alignas(16) GPack {

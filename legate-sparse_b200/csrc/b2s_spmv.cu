@@ -1,4 +1,4 @@
-// b2s_spmv.cu — CSR SpMV for sm_100a.
+// b2s_spmv.cu — CSR SpMV for sm_90a.
 //
 // Replaces CSRSpMVRowSplit (reference src/sparse/array/csr/spmv.cu:30-163 = one cusparseSpMV
 // call; CPU semantics spmv.cc:36-43: y[i] = sum_j vals[j] * x[crd[j]]).
@@ -392,25 +392,19 @@ static int launch_pipe_inst(const PlanHeader* P, const int64_t* indptr, const I*
     max_blocks_per_sm[dev].store(nb_max, std::memory_order_release);
   }
   // Resident CTAs / ring depth / shared-memory carve-out (a per-LAUNCH attribute) of the products
-  // consumer, measured on C2 (random, column-blocked), the 4096^2 Laplacian and the power-law matrix
-  // (profiles/r2_occ_sweep.txt, r2_occ_sweep2.txt; 1024-nnz tiles, ms):
-  //   3-stage ring, 3 CTAs/SM (130 KB of shared memory, carve-out 57 %, L1 = 124 KB): 2.13 / 0.277 / 0.534
-  //   3-stage ring, 4 CTAs/SM (174 KB, carve-out 80 %, L1 = 60 KB)                  : 2.24 / 0.245 / 0.573
-  //   4-stage ring, 3 CTAs/SM (173 KB, carve-out 80 %)                              : 2.20 / 0.275 / 0.568
-  //   4-stage ring, 2 CTAs/SM (carve-out 55 %)                                      : 2.32 / 0.357 / 0.505
-  //   2-stage ring, 3 CTAs/SM (carve-out 44 %)                                      : 2.60 / 0.364 / 0.488
-  // Round 1 ran 2 CTAs: its gathers allocated L1 lines and a third CTA cost more L1 than it hid
-  // latency.  With L1::no_allocate gathers the third CTA wins and 3 stages leave it the large L1.
-  // L1-friendly matrices (near tiles: the gathers hit L1) take the fourth CTA.  The long-row
-  // (power-law) instances run the shallow ring: their gathers miss L2 19 % of the time and the
-  // larger L1 (= more requests in flight) matters more there than prefetch depth.
+  // consumer (1024-nnz tiles):
+  //   3-stage ring, 3 CTAs/SM (130 KB of shared memory, carve-out 57 %, L1 = 124 KB): C2, the Laplacian
+  //   2-stage ring, 3 CTAs/SM (carve-out 50 %)                                      : long-row (power-law)
+  // Swept on an H100 SXM (700 W) with tools/launch_sweep.py, ms per SpMV: C2 (column-blocked)
+  // 3 CTAs 4.86, 2 CTAs 4.90, 3 CTAs at 80 % 4.91, 4 CTAs at 80 % 4.94; the Laplacian 3 CTAs 0.516,
+  // 4 CTAs at 80 % 0.531; the power-law matrix (long-row pass) 3 CTAs 1.707, 3 CTAs at 80 % 1.742.
+  // The shallow ring leaves the long-row instances the larger L1 (= more requests in flight).
   // B2S_SPMV_CARVEOUT (percent) / B2S_SPMV_CTAS override for sweeps.
   const int l1_alloc = env_int("B2S_SPMV_L1_ALLOC", P->near_tiles * 2 >= P->ntiles ? 1 : 0) != 0;
   int carve = -1, cap = 0;
   if (!WINDOW) {
-    if (LONGROWS)                    { cap = 3; carve = 50; }
-    else if (l1_alloc && TILE == 1024) { cap = 4; carve = 80; }
-    else                             { cap = 3; carve = TILE == 1024 ? 57 : 80; }
+    if (LONGROWS) { cap = 3; carve = 50; }
+    else          { cap = 3; carve = TILE == 1024 ? 57 : 80; }
   }
   carve = env_int("B2S_SPMV_CARVEOUT", carve);
   cap = env_int("B2S_SPMV_CTAS", cap);
@@ -486,12 +480,11 @@ static int launch_pipe_tile(const PlanHeader* P, const int64_t* indptr, const I*
   bool longrows = P->max_row > 64 && P->max_row * P->nrows > 8 * P->nnz;
   longrows = env_int("B2S_SPMV_LONGROWS", longrows ? 1 : 0) != 0;
   if constexpr (!DOT && TILE == 1024 && sizeof(V) <= 8) {
-    // skewed rows: the async-gather kernel (segmented sum, next tile's gathers in flight during the
-    // reduction).  B2S_SPMV_AGATHER=0 falls back to the long-row pass of the products consumer, =1 forces
-    // the kernel for every gathered (non-window) matrix.
-    const int ag = env_int("B2S_SPMV_AGATHER", -1);
+    // the async-gather kernel (segmented sum, next tile's gathers in flight during the reduction) on
+    // request only (B2S_SPMV_AGATHER=1, every gathered, non-window matrix): on an H100 the long-row
+    // pass of the products consumer is faster on the power-law matrix (1.707 vs 1.762 ms).
     if (!bcast && P->max_tile_rows <= 65535 && P->nrows > 0 && (uintptr_t)x % 16 == 0 &&
-        (ag == 1 || (ag != 0 && longrows))) {
+        env_int("B2S_SPMV_AGATHER", 0) == 1) {
       return launch_agather_inst<V, I>(P, indptr, cols, vals, x, y, npartials, accumulate, st);
     }
   }
@@ -704,7 +697,7 @@ int plan_create_impl(b2s_itype it, int64_t nrows, int64_t ncols, int64_t nnz,
   P->it = it; P->nrows = nrows; P->ncols = ncols; P->nnz = nnz;
   // Tile size: an explicit B2S_SPMV_TILE_NNZ wins; otherwise plan with 2048-nnz tiles first and,
   // when the matrix is not window-friendly (x gathers must go to L2), re-plan with 1024-nnz tiles
-  // (the configuration each consumer flavour measured fastest with on B200).
+  // (the configuration each consumer flavour measured fastest with).
   const bool forced = getenv("B2S_SPMV_TILE_NNZ") != nullptr || force_tile > 0;
   int64_t candidates[2] = {getenv("B2S_SPMV_TILE_NNZ") ? default_tile_nnz() : (force_tile > 0 ? force_tile : 2048), 1024};
   for (int attempt = 0; attempt < 2; ++attempt) {

@@ -6,17 +6,16 @@
 // spmv_fixup_kernel in tile order; no floating-point atomics, bit-reproducible), different consumer:
 //
 //   * the x gathers are cp.async (LDGSTS) copies from global memory STRAIGHT INTO SHARED MEMORY
-//     (tools/gather_paths: the same 0.94 requests/clk/SM as a register load, but no destination
-//     register is held while the request is in flight).  They are the L1-BYPASSING 16-byte form
+//     (the same request path as a register load, but no destination register is held while the
+//     request is in flight).  They are the L1-BYPASSING 16-byte form
 //     (cp.async.cg, SASS LDGSTS.E.BYPASS.128: the aligned 16 bytes that hold x[col]; the reduction picks
 //     its half): the 4/8-byte form exists only as .ca, which pins an L1 line per request in flight — with
-//     the L1 that is left beside ~200 KB of shared memory that capped the kernel at 0.21 gathers/clk/SM
-//     (1.15 ms on config 5 whatever the occupancy).  A thread gathers exactly the 4 elements it
+//     the L1 that is left beside ~200 KB of shared memory that caps the gather rate whatever the
+//     occupancy.  A thread gathers exactly the 4 elements it
 //     reduces later, so completion is a per-thread cp.async.wait_group — no barrier.  The gathers of
 //     tile i+1 are issued BEFORE tile i is reduced: the whole reduction of a tile overlaps the L2 /
-//     DRAM latency of the next one.  (The products consumer of spmv_pipe_kernel spent 29 % of its time
-//     with gathers in flight on this matrix class and the rest in its reduction passes with nothing
-//     outstanding — profiles/r2_phase_timing.txt.)
+//     DRAM latency of the next one.  (The products consumer of spmv_pipe_kernel spends most of its
+//     time on this matrix class in reduction passes with no gather outstanding.)
 //   * the reduction is a SEGMENTED SUM in nnz order: a thread owns 4 consecutive products
 //     (val * x read back from shared memory), rows are delimited by per-element row-start marks, rows
 //     that end inside a thread are stored at once, open pieces are combined by a warp-level segmented
@@ -27,8 +26,7 @@
 //   * the column ids and values of a tile are read by the thread that uses them (16 / 32 coalesced bytes,
 //     ld.global.nc.L1::no_allocate, L2 evict_first) one tile AHEAD into registers: staging them in
 //     shared memory as spmv_pipe_kernel does left too little of it for the 16 bytes per element the
-//     gathers need (3 CTAs x 1-2 tiles of TMA in flight could not cover the DRAM latency: consumers
-//     waited 23 % of the time for values).  Shared memory holds only the gathered x (2 tiles), the
+//     gathers need (3 CTAs x 1-2 tiles of TMA in flight could not cover the DRAM latency).  Shared memory holds only the gathered x (2 tiles), the
 //     row-start marks (4 tiles) and the row pointers (4 tiles): 53 KB, 4 CTAs per SM.
 //   * a ROW-POINTER WARP does everything that needs indptr: lane 0 fetches the tile's slice of
 //     indptr with a TMA bulk copy (4 tiles ahead); then all 32 lanes turn it into row-start marks

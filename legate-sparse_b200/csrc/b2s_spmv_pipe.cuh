@@ -4,7 +4,7 @@
 // tiles from the plan; the tile where a row starts owns y[r]; later pieces go to head[t] and
 // are added by spmv_fixup_kernel in tile order), different execution structure:
 //
-//   * persistent CTAs (grid = resident CTAs per SM x 148), tiles handed out round-robin;
+//   * persistent CTAs (grid = resident CTAs per SM x number of SMs), tiles handed out round-robin;
 //   * one PRODUCER warp: an elected lane fills a STAGES-deep shared-memory ring with TMA bulk
 //     copies (cp.async.bulk … mbarrier::complete_tx, SASS UBLKCP) of the tile's contiguous
 //     slices: col indices, values, the indptr entries of the tile's rows and — when the plan
@@ -27,7 +27,7 @@
 namespace b2s {
 
 #ifdef B2S_PIPE_TIMING
-// phase cycle counters of consumer group 0 / thread 0 of CTA 0 (debug builds only, tools/gpu_r2_timing.sh)
+// phase cycle counters of consumer group 0 / thread 0 of CTA 0 (debug builds with -DB2S_PIPE_TIMING only)
 __device__ unsigned long long g_pipe_phase[16];
 #define B2S_T(k) do { if (blockIdx.x == 0 && tid == 0) { const long long _n = clock64(); g_pipe_phase[k] += (unsigned long long)(_n - _tprev); _tprev = _n; } } while (0)
 #else
@@ -92,12 +92,12 @@ template <typename I, int C> struct alignas((sizeof(I) * C) < 16 ? (sizeof(I) * 
 // WINDOW also selects the consumer: window matrices (banded / stencil) use the row-walk consumer,
 // all others the products consumer (each measured fastest there; the cross combinations were never
 // faster and are not instantiated).  BCAST compiles the peer stores in; the plain instances carry
-// no trace of them (the peer ranges cost the banded kernel 13% when they were a runtime branch).
+// no trace of them (as a runtime branch the peer ranges slowed the banded kernel).
 // NG = consumer groups of the products consumer (1 or 2; tile i of the CTA uses ring stage i % STAGES and
 // is consumed by group i % NG, whose GT threads are the arrivals its "empty" barrier expects).
 // LONGROWS (products consumer, skewed row lengths — power-law matrices): rows of the tile longer than
 // 32 x (lanes per row) are not summed by their small lane group (one lane walking a 1000-entry row
-// stalls its whole group at the next barrier: 41 % barrier stalls on BASELINE config 5) but
+// stalls its whole group at the next barrier) but
 // deferred to a second pass where each gets a full warp.
 template <typename V, typename I, int TILE, int STAGES, bool WINDOW, bool DOT, bool BCAST, int NG, bool LONGROWS = false>
 __global__ void __launch_bounds__(kPipeThreads, (WINDOW || sizeof(V) > 8) ? 0 : (LONGROWS ? 3 : 4))   // products: 4 (long rows: 3) CTAs/SM must fit the register file
@@ -273,12 +273,10 @@ spmv_pipe_kernel(int64_t nrows, int64_t ncols, int64_t nnz, int64_t ntiles,
       }
       B2S_T(2);
       if (meta.full_tile) {
-        // Gathers are issued in batches of BCH chunks = 4 gathers per thread.  Measured on the
-        // column-blocked C2 matrix (profiles/r2_pipe_sweep.txt): all 8 of a thread at once 2.40 ms,
-        // 4 at a time 2.29 ms, 2 at a time 2.41 ms; with L1::no_allocate on the gathers (their L1
-        // hit rate is 0.5 %, so a line per outstanding request buys nothing) 2.23 ms.  Matrices
-        // whose tiles keep re-touching a small range of x (the 4096^2 Laplacian: 8 K elements per
-        // tile) want the opposite: with no_allocate their SpMV went from 0.276 to 0.349 ms, so the
+        // Gathers are issued in batches of BCH chunks = 4 gathers per thread (fastest of 2 / 4 / 8 on
+        // the column-blocked C2 matrix), with L1::no_allocate: random gathers almost never hit L1,
+        // so a line per outstanding request buys nothing.  Matrices whose tiles keep re-touching a
+        // small range of x (the 4096^2 Laplacian: 8 K elements per tile) want the opposite, so the
         // plan's "near tiles" statistic selects the allocating load for them (flag bit 1).
         constexpr int BCH = (4 / C) > 0 ? ((4 / C) < NCH ? (4 / C) : NCH) : 1;
         static_assert(NCH % BCH == 0, "chunks per thread must be a multiple of the gather batch");
@@ -390,8 +388,8 @@ spmv_pipe_kernel(int64_t nrows, int64_t ncols, int64_t nnz, int64_t ntiles,
       rb1 = rb2; rl1 = rl2;   // rotate at the END of the tile: the plan loads issued at its top have landed
       // the product stores above are generic-proxy writes to memory the TMA refills later: the
       // cross-proxy fence is issued ONCE, by the producer, after it has acquired this arrival
-      // (fence.proxy.async = MEMBAR.ALL.CTA + FENCE.VIEW.ASYNC: 4 % of the kernel when all 256
-      // consumer threads executed it per tile)
+      // (fence.proxy.async = MEMBAR.ALL.CTA + FENCE.VIEW.ASYNC: measurable when all 256 consumer
+      // threads executed it per tile)
       mbar_arrive(&empty_bar[s]);
     }
     if (DOT) {

@@ -10,7 +10,7 @@
 namespace b2s {
 
 constexpr int kVecThreads   = 256;
-constexpr int kMaxRedBlocks = kNumSMs * 8;  // 1184
+constexpr int kMaxRedBlocks = kNumSMs * 8;
 
 template <typename V> struct alignas(16) Pack {
   static constexpr int N = (16 / sizeof(V)) > 0 ? (16 / sizeof(V)) : 1;

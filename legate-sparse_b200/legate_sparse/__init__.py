@@ -1,8 +1,8 @@
-"""legate_sparse — the B200-native drop-in for the nv-legate/legate-sparse Python surface.
+"""legate_sparse — the H100-native drop-in for the nv-legate/legate-sparse Python surface.
 
-Same names as the reference package (/root/reference legate_sparse/__init__.py:22-29):
+Same names as the reference package (reference legate_sparse/__init__.py:22-29):
 ``csr_array``/``csr_matrix``, ``dia_array``, ``diags``, ``random``, ``mmread``, ``linalg`` …, but every
-SpMV / SpGEMM / CG vector operation is a hand-written sm_100a CUDA kernel in
+SpMV / SpGEMM / CG vector operation is a hand-written sm_90a CUDA kernel in
 ``libb200sparse.so`` reached through a plain C ABI (include/b200sparse.h).  No Legate,
 no cuSPARSE, no CPU fallback.
 """

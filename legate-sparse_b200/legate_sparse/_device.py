@@ -49,7 +49,7 @@ def vt_enum(dt) -> int:
     try:
         return _NP2ENUM[np.dtype(dt)]
     except KeyError:
-        raise NotImplementedError(f"dtype {dt} is not supported by the B200 kernels")
+        raise NotImplementedError(f"dtype {dt} is not supported by the native kernels")
 
 
 def real_dtype(dt) -> np.dtype:
@@ -67,7 +67,7 @@ def require_cuda() -> torch.device:
         N.load()
         if not torch.cuda.is_available():
             raise RuntimeError(
-                "legate_sparse (b200): no CUDA device is available; the sm_100a kernels are the "
+                "legate_sparse (b200): no CUDA device is available; the sm_90a kernels are the "
                 "only compute path (there is no CPU fallback)."
             )
         _checked = True
@@ -191,7 +191,7 @@ def _side_stream():
 class ColBlock:
     """Owner of a native b2s_colblock (column-blocked copy of a row block) + its workspace.
 
-    Built when ``suggest`` says the gathers of x have no L2 locality (x much larger than ~40 MB and
+    Built when ``suggest`` says the gathers of x have no L2 locality (x much larger than ~20 MB and
     rows reaching across it); holds a copy of the values, so it is cached with the row block and
     dropped whenever the matrix data changes."""
 

@@ -1,7 +1,7 @@
 """ctypes binding of libb200sparse.so (the C ABI declared in include/b200sparse.h).
 
 This replaces the reference's cffi loader + Legate task launch
-(/root/reference legate_sparse/config.py:49-88, runtime.py:96-103): there the
+(reference legate_sparse/config.py:49-88, runtime.py:96-103): there the
 only exported C symbol is ``legate_sparse_perform_registration`` and every
 operation travels through a Legate ``TaskContext``; here every operation is a
 plain ``extern "C"`` call on raw device pointers.

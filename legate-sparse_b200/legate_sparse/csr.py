@@ -1,8 +1,8 @@
 """csr_array — the scipy.sparse-shaped CSR matrix of the reference
-(/root/reference legate_sparse/csr.py:88-558) on top of the B200 kernels.
+(reference legate_sparse/csr.py:88-558) on top of the native kernels.
 
 Hot path (SURVEY §8a): ``dot``/``@`` → :func:`spmv` (csr.py:562-593 upstream) or
-:func:`spgemm_csr_csr_csr` (csr.py:598-748 upstream) → C ABI → sm_100a kernels.
+:func:`spgemm_csr_csr_csr` (csr.py:598-748 upstream) → C ABI → sm_90a kernels.
 
 Storage differs from the reference on purpose: plain ``indptr`` (int64) instead of the
 Rect<1> ``pos`` store, column indices narrowed to int32 on the device when
@@ -899,7 +899,7 @@ def _bcast_ok(blk: _RowBlock) -> bool:
 
 def spmv(A: csr_array, x, y=None):
     """y = A @ x.  Replaces the reference's ``spmv`` task launch (csr.py:562-593): the row
-    block of this rank is computed by the sm_100a kernel; with more than one rank the blocks
+    block of this rank is computed by the sm_90a kernel; with more than one rank the blocks
     are all-gathered so that y is replicated like x.
 
     numpy in → numpy out (H2D of x, D2H of y); CUDA tensor in → CUDA tensor out."""

@@ -2,13 +2,13 @@
 gloo in CPU tests).
 
 The reference has exactly one strategy (SURVEY §2b): Legate tiles the rows of A equally over
-the processors (``align(y, pos)``, /root/reference legate_sparse/csr.py:587-591), each GPU
+the processors (``align(y, pos)``, reference legate_sparse/csr.py:587-591), each GPU
 gets the contiguous crd/vals slice of its rows and the x window it needs; the only NCCL call
 upstream is a 1-element all-gather of per-GPU nnz (spgemm_csr_csr_csr.cu:43-62).
 
 Here: every rank runs the same script (SPMD).  A matrix is split into row blocks
 ``bounds[r] .. bounds[r+1]``; x is replicated; each rank computes its block of y with the
-local sm_100a kernel and — when a replicated result is needed (CG/GMRES) — the blocks are
+local sm_90a kernel and — when a replicated result is needed (CG/GMRES) — the blocks are
 all-gathered (NCCL over NVLink / NVSwitch).  Dense-vector reductions are done on the local
 block and all-reduced.
 """

@@ -1,5 +1,5 @@
 """Iterative solvers and the LinearOperator family
-(reference /root/reference legate_sparse/linalg.py:85-668).
+(reference legate_sparse/linalg.py:85-668).
 
 The solver loops keep every vector in HBM as a CUDA tensor and every scalar (rho, pq, …) as
 a 1-element device array, exactly like the reference keeps them as Legate futures
@@ -758,7 +758,7 @@ def gmres(
 ):
     """Restarted GMRES with classical Gram-Schmidt (reference linalg.py:540-668, itself the
     CuPy algorithm).  Returns ``(x, info)``.  SpMV, norms and the tall-skinny
-    ``V^H u`` / ``u -= V h`` / ``x += V y`` products run on the B200 kernels (b2s_cgs_project /
+    ``V^H u`` / ``u -= V h`` / ``x += V y`` products run on the native kernels (b2s_cgs_project /
     b2s_cgs_update / b2s_vscale_inv; the basis is stored basis-vector-major); the
     (restart+1) x restart least-squares problem is solved on the host, as upstream."""
     from . import _device as D

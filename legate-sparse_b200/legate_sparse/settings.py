@@ -9,9 +9,9 @@ only kernel-selection switches survive here — the Legate settings machinery is
                               aligned, else tile, else rowvec)
   B2S_SPMV_TILE_NNZ=1024|2048|4096   (read by the native library)
   B2S_SPMV_LONGROWS=0|1              (read by the native library) force the long-row pass off / on
-  B2S_SPMV_AGATHER=0|1               (read by the native library) skewed row lengths: 0 keeps the products
-                                     consumer (+ long-row pass), 1 forces the async-gather kernel for every
-                                     gathered matrix on 1024-nnz tiles (default: chosen from the plan statistics)
+  B2S_SPMV_AGATHER=0|1               (read by the native library) 1 runs the async-gather kernel for every
+                                     gathered matrix on 1024-nnz tiles; default 0: the products consumer
+                                     (+ long-row pass for skewed row lengths)
   B2S_SPMV_CTAS=N, B2S_SPMV_CARVEOUT=P   (read by the native library) resident CTAs per SM / shared-memory
                                      carve-out of the pipe and async-gather kernels (sweeps)
   B2S_SPMV_NO_WINDOW=1               (read by the native library) disable TMA x-window staging

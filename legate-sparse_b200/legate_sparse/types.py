@@ -1,7 +1,7 @@
 """Index / count dtypes of the public surface.
 
 The reference fixes column coordinates to int64 and non-zero counts to uint64
-(/root/reference legate_sparse/types.py:20-25); user-visible index arrays keep those types here
+(reference legate_sparse/types.py:20-25); user-visible index arrays keep those types here
 (the device kernels may narrow columns to int32, see csr.py)."""
 import numpy as _np
 

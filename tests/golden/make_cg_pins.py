@@ -1,17 +1,18 @@
 #!/usr/bin/env python
 """Pins for BASELINE config 3 (CG on the 5-point Laplacian, rtol 1e-10): run
 ``scipy.sparse.linalg.cg`` — the oracle north_star names — AND the reference's own ``linalg.cg``
-(/root/reference legate_sparse/linalg.py:465-535, imported unmodified behind the shims of
+(reference legate_sparse/linalg.py:465-535, imported unmodified behind the shims of
 make_golden.py) on Poisson N x N grids, and record what a GPU run can be held to without
 shipping the 8-33 MB iterates: iteration counts, TRUE relative residuals ||b - A x|| / ||b||,
 ||x||, and a strided sample of x.
 
-    python tests/golden/make_cg_pins.py [1024 2048]      → tests/golden/scipy_cg_poisson.npz
+    LEGATE_SPARSE_REFERENCE=<reference checkout> python tests/golden/make_cg_pins.py [1024 2048]
+                                                         → tests/golden/scipy_cg_poisson.npz
 
 Both solvers stop on the RECURRENCE residual; after thousands of iterations the true residual
 has drifted above it (1024^2: 4.7e-10 for a 1e-10 request, for scipy and the reference alike) —
 the pins record the true figures of both so that the GPU solve is compared like for like.
-Run time in the build container (8 cores): 1024^2 ~2.5 min, 2048^2 ~20 min.
+Run time on 8 host cores: 1024^2 ~2.5 min, 2048^2 ~20 min.
 """
 import os
 import sys

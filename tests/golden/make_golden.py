@@ -1,9 +1,9 @@
 #!/usr/bin/env python
-"""Generate the golden fixtures under tests/golden/.  Run ONLY in the build container
-(needs /root/reference); the fixtures it writes are committed and are what the tests read —
-nothing under tests/ touches /root/reference at test time.
+"""Generate the golden fixtures under tests/golden/.  Needs a checkout of the reference
+(nv-legate/legate-sparse), named by LEGATE_SPARSE_REFERENCE; the fixtures it writes are committed
+and are what the tests read — nothing under tests/ touches the reference at test time.
 
-    python tests/golden/make_golden.py
+    LEGATE_SPARSE_REFERENCE=<reference checkout> python tests/golden/make_golden.py
 
 What it produces
   reference_known_answers.json  known-answer vectors transcribed from the reference's own
@@ -17,7 +17,7 @@ What it produces
 
 How the reference's Python runs here: `legate` and `cupynumeric` are not installable
 (SURVEY F13), so this script registers SHIMS before importing the reference modules
-*unmodified* from /root/reference/legate_sparse: cupynumeric → numpy, legate.core → a stub
+*unmodified* from the reference's legate_sparse/: cupynumeric → numpy, legate.core → a stub
 namespace, legate_sparse.{config,runtime,utils,csr} → minimal stand-ins (stores are plain
 numpy arrays; csr_array just records the arrays it is given).  The Legate TASK launched by
 linalg.cg_axpby is replaced by the C restatement of its body (oracle.axpby,
@@ -37,7 +37,7 @@ import scipy.stats as stats
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.normpath(os.path.join(HERE, "..", ".."))
-REF = "/root/reference"
+REF = os.environ.get("LEGATE_SPARSE_REFERENCE", "")
 sys.path.insert(0, ROOT)
 from oracle import oracle  # noqa: E402
 
@@ -108,6 +108,8 @@ def install_shims():
 
 
 def ref_modules():
+    if not os.path.isdir(os.path.join(REF, "legate_sparse")):
+        sys.exit("set LEGATE_SPARSE_REFERENCE to a checkout of nv-legate/legate-sparse")
     install_shims()
     gallery = importlib.import_module("legate_sparse.gallery")
     linalg = importlib.import_module("legate_sparse.linalg")

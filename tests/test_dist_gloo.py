@@ -1,6 +1,6 @@
 """world_size-2 gloo tests (CPU) of the N>1 host-side logic: row partitions, ragged all-gather,
 the distributed SpMV assembly and the all-gather(v) of SpGEMM blocks.  The per-rank block
-product is computed with the ORACLE here (the sm_100a kernel needs a GPU) — what is under
+product is computed with the ORACLE here (the sm_90a kernel needs a GPU) — what is under
 test is the partition + collective plumbing of legate_sparse.dist."""
 import os
 import socket

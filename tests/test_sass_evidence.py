@@ -1,4 +1,4 @@
-"""Build-artifact checks that need no GPU: the shipped libb200sparse.so carries sm_100a SASS with the
+"""Build-artifact checks that need no GPU: the shipped libb200sparse.so carries sm_90a SASS with the
 instruction forms DESIGN.md claims for the SpMV hot path (SURVEY §8 row a3) — TMA bulk copies and mbarrier
 traffic in the pipe kernel, L1-bypassing 16-byte cp.async gathers in the async-gather kernel — and none of
 the LDGSTS mis-encoding ptxas 12.9 produced for one variant of that kernel (see csrc/Makefile)."""
@@ -30,8 +30,8 @@ def functions(sass_text):
     return {p.split("\n", 1)[0].strip(): p for p in parts[1:]}
 
 
-def test_sass_is_sm100a_and_has_the_claimed_instruction_forms(sass):
-    assert "sm_100a" in sass
+def test_sass_is_sm90a_and_has_the_claimed_instruction_forms(sass):
+    assert "sm_90a" in sass
     fn = functions(sass)
     pipe = [t for n, t in fn.items() if "spmv_pipe_kernel" in n]
     ag = [t for n, t in fn.items() if "spmv_agather_kernel" in n]

@@ -1,5 +1,5 @@
 // tools/gather_paths.cu — which on-chip path can gather 8-byte elements of an L2-resident vector
-// fastest on sm_100a?  Standalone micro-benchmark (no torch, no libb200sparse) behind the claim in
+// fastest on sm_90a?  Standalone micro-benchmark (no torch, no libb200sparse) behind the claim in
 // DESIGN.md §3.1b that config-2 SpMV (uniformly random columns) is bound by the per-request rate of
 // the gather path and not by HBM.  Every mode performs the SAME work: for `nnz` random int32 column
 // ids (read once from HBM, 4 B each) fetch x[col] (fp64) from an x of `xmb` MB and add it up; modes
@@ -7,11 +7,9 @@
 //
 //   lsu        ld.global.nc.f64 per element (what spmv_pipe_kernel's products consumer does)
 //   lsu16      ld.global.nc.v2.f64 of the aligned 16-byte pair holding the element
-//   g4         TMA tile::gather4 (UTMALDG.2D.GATHER4) on x viewed as a [ncols/2][2] fp64 tensor:
-//              one instruction fetches four 16-byte rows into shared memory; consumers read them
 //   bulk16     one 16-byte cp.async.bulk (UBLKCP) per element
-//   mix        8 LSU warps gather (2048-TM) elements of every 2048-element tile themselves while a
-//              producer warp stages the other TM through gather4 — both request paths at once
+//   mixb16     8 LSU warps gather (2048-TM) elements of every 2048-element tile themselves while a
+//              producer warp stages the other TM through bulk16 — both request paths at once
 //   ldgsts     cp.async.ca.shared.global 8-byte gathers (LDGSTS): the LSU request path, but the data lands in
 //              shared memory without holding a destination register while in flight
 //   dsmem      x slice spread over the shared memory of a thread-block cluster (8 or 16 CTAs),
@@ -19,9 +17,8 @@
 //
 // Output: G gathers/s per mode + gathers per clock per SM (at the SM clock measured in-kernel),
 // and a checksum against the lsu mode.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -lineinfo tools/gather_paths.cu -o tools/gather_paths
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -lineinfo tools/gather_paths.cu -o tools/gather_paths
 // Usage: gather_paths [xmb=40] [nnz_millions=256] [iters=5]
-#include <cuda.h>
 #include <cuda_runtime.h>
 #include <cstdint>
 #include <cstdio>
@@ -69,12 +66,6 @@ __device__ __forceinline__ bool mbar_wait(uint64_t* bar, uint32_t phase, int* er
   for (int i = 0; i < (1 << 20); ++i) if (mbar_try(bar, phase)) return true;
   atomicExch(err, 1);
   return false;
-}
-__device__ __forceinline__ void tma_gather4(void* dst, const CUtensorMap* tm, int r0, int r1, int r2, int r3, uint64_t* bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.tile::gather4.mbarrier::complete_tx::bytes "
-      "[%0], [%1, {%2, %3, %4, %5, %6}], [%7];" ::"r"(smem_u32(dst)), "l"(tm), "r"(0), "r"(r0), "r"(r1), "r"(r2), "r"(r3),
-      "r"(smem_u32(bar)) : "memory");
 }
 __device__ __forceinline__ void bulk16(void* dst, const void* src, uint64_t* bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], 16, [%2];"
@@ -217,17 +208,17 @@ __global__ void __launch_bounds__(256) k_ldgsts(int64_t nnz, const int* __restri
   block_sum_to(acc, out);
 }
 
-// ---------------------------------------------------------------- TMA gather4 / bulk16 (optionally mixed with LSU gathers)
+// ---------------------------------------------------------------- bulk16 (optionally mixed with LSU gathers)
 // CTA = NCW consumer warps + 1 producer warp.  A tile = 2048 consecutive column ids.  The LAST TM of
 // them are fetched by the producer warp into a ring stage (TM*16 bytes: every element arrives as the
 // aligned 16-byte pair that holds it) together with the tile's TM column ids; consumers read them
 // out of shared memory.  The first 2048-TM are gathered by the consumers through the LSU.
-template <int NCW, int TILE, int TM, int STAGES, bool BULK16>
+template <int NCW, int TILE, int TM, int STAGES>
 __global__ void __launch_bounds__((NCW + 1) * 32)
-k_tma(const __grid_constant__ CUtensorMap tmap, int64_t ntiles, const int* __restrict__ cols, const double* __restrict__ x,
+k_tma(int64_t ntiles, const int* __restrict__ cols, const double* __restrict__ x,
       double* out, int consume, int* err) {
   constexpr int NCT = NCW * 32;
-  constexpr int SLOT = BULK16 ? 16 : 32;   // bytes per element: gather4 needs a 128-byte aligned destination (4 x 16 B used)
+  constexpr int SLOT = 16;   // bytes per element
   constexpr int STAGE_BYTES = TM * SLOT + TM * 4;
   extern __shared__ __align__(128) unsigned char smem[];
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)STAGE_BYTES * STAGES);
@@ -263,14 +254,10 @@ k_tma(const __grid_constant__ CUtensorMap tmap, int64_t ntiles, const int* __res
 #pragma unroll
       for (int q = 0; q < TM / 128; ++q) {
         unsigned char* dst = st + (size_t)(q * 128 + lane * 4) * SLOT;
-        if (BULK16) {
-          bulk16(dst, x + (c[q].x & ~1), &full[s]);
-          bulk16(dst + 16, x + (c[q].y & ~1), &full[s]);
-          bulk16(dst + 32, x + (c[q].z & ~1), &full[s]);
-          bulk16(dst + 48, x + (c[q].w & ~1), &full[s]);
-        } else {
-          tma_gather4(dst, &tmap, c[q].x >> 1, c[q].y >> 1, c[q].z >> 1, c[q].w >> 1, &full[s]);
-        }
+        bulk16(dst, x + (c[q].x & ~1), &full[s]);
+        bulk16(dst + 16, x + (c[q].y & ~1), &full[s]);
+        bulk16(dst + 32, x + (c[q].z & ~1), &full[s]);
+        bulk16(dst + 48, x + (c[q].w & ~1), &full[s]);
       }
     }
     return;
@@ -305,21 +292,6 @@ k_tma(const __grid_constant__ CUtensorMap tmap, int64_t ntiles, const int* __res
     }
   }
   block_sum_to(acc, out);
-}
-
-// one gather4 with known rows: what lands where?  (validates the tensor-map box convention)
-__global__ void k_g4_probe(const __grid_constant__ CUtensorMap tmap, int r0, int r1, int r2, int r3, double* out, int* err) {
-  __shared__ __align__(128) double buf[16];
-  __shared__ uint64_t bar;
-  for (int i = 0; i < 16; ++i) buf[i] = -1.0;
-  mbar_init(&bar, 1);
-  asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  mbar_expect_tx(&bar, 64);
-  tma_gather4(buf, &tmap, r0, r1, r2, r3, &bar);
-  bool ok = mbar_wait(&bar, 0, err);
-  for (int i = 0; i < 16; ++i) out[i] = buf[i];
-  out[16] = ok ? 1.0 : 0.0;
 }
 
 // ---------------------------------------------------------------- DSMEM
@@ -379,11 +351,8 @@ struct Timer {
   float stop() { cudaEventRecord(b); cudaEventSynchronize(b); float ms; cudaEventElapsedTime(&ms, a, b); return ms; }
 };
 
-typedef CUresult (*EncodeTiled_t)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static double g_mhz = 1965.0;
+static double g_mhz = 1000.0;   // replaced by the in-kernel measurement
+static int g_sms = 1;
 static double* d_out;
 static int* d_err;
 static double ref_sum = 0;
@@ -393,7 +362,7 @@ static void report(const char* name, float ms, int64_t nnz, double sum, double e
   double rate = nnz / (ms * 1e-3) / 1e9;
   double rel = expect > 0 ? fabs(sum - expect) / fabs(expect) : 0;
   printf("%-44s %8.3f ms  %7.1f Ggather/s  %5.2f /clk/SM   checksum relerr %.1e%s\n", name, ms, rate,
-         rate * 1e9 / (g_mhz * 1e6) / 148.0, rel, err ? "  [TIMEOUT FLAG SET]" : "");
+         rate * 1e9 / (g_mhz * 1e6) / g_sms, rel, err ? "  [TIMEOUT FLAG SET]" : "");
   fflush(stdout);
   CK(cudaMemset(d_err, 0, 4));
 }
@@ -414,47 +383,48 @@ static void run(const char* name, int64_t nnz, int iters, double expect, F launc
   if (expect == 0 && ref_sum == 0) ref_sum = sum;
 }
 
-template <int NCW, int TILE, int TM, int STAGES, bool BULK16>
-static void run_tma(const char* label, const CUtensorMap& tm, int64_t nnz, const int* cols, const double* x, int iters, int ctas_per_sm,
+template <int NCW, int TILE, int TM, int STAGES>
+static void run_tma(const char* label, int64_t nnz, const int* cols, const double* x, int iters, int ctas_per_sm,
                     int consume, double expect) {
-  auto kern = k_tma<NCW, TILE, TM, STAGES, BULK16>;
-  size_t smem = (size_t)(TM * ((BULK16 ? 16 : 32) + 4)) * STAGES + 16 * STAGES + 128;
+  auto kern = k_tma<NCW, TILE, TM, STAGES>;
+  size_t smem = (size_t)(TM * (16 + 4)) * STAGES + 16 * STAGES + 128;
   CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int occ = 0; CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, (NCW + 1) * 32, smem));
   int per = ctas_per_sm < occ ? ctas_per_sm : occ;
   int64_t ntiles = nnz / TILE;
   char name[128];
   snprintf(name, sizeof name, "%s TMA %d of %d, warps=%d+1, CTAs/SM=%d%s", label, TM, TILE, NCW, per, consume ? "" : " (no read-out)");
-  run(name, ntiles * TILE, iters, consume ? expect : -1.0, [&] { kern<<<per * 148, (NCW + 1) * 32, smem>>>(tm, ntiles, cols, x, d_out, consume, d_err); });
+  run(name, ntiles * TILE, iters, consume ? expect : -1.0, [&] { kern<<<per * g_sms, (NCW + 1) * 32, smem>>>(ntiles, cols, x, d_out, consume, d_err); });
 }
 
 int main(int argc, char** argv) {
   int xmb = argc > 1 ? atoi(argv[1]) : 40;
   int64_t nnz = (int64_t)(argc > 2 ? atoi(argv[2]) : 256) << 20;
   int iters = argc > 3 ? atoi(argv[3]) : 5;
-  nnz = nnz / (2048 * 148 * 8) * (2048 * 148 * 8);
-  int64_t ncols = ((int64_t)xmb << 20) / 8;
   cudaDeviceProp prop; CK(cudaGetDeviceProperties(&prop, 0));
+  g_sms = prop.multiProcessorCount;
+  nnz = nnz / (2048 * g_sms * 8) * (2048 * g_sms * 8);
+  int64_t ncols = ((int64_t)xmb << 20) / 8;
   printf("device %s, %d SMs, L2 %d MB; x = %d MB (%lld fp64), %lld gathers per pass\n", prop.name, prop.multiProcessorCount,
          prop.l2CacheSize >> 20, xmb, (long long)ncols, (long long)nnz);
   int* cols; double* x; double* d_mhz;
   CK(cudaMalloc(&cols, nnz * 4)); CK(cudaMalloc(&x, ncols * 8)); CK(cudaMalloc(&d_out, 64 * 8)); CK(cudaMalloc(&d_err, 4));
   CK(cudaMalloc(&d_mhz, 8)); CK(cudaMemset(d_err, 0, 4));
-  gen_cols<<<148 * 8, 256>>>(nnz, ncols, cols);
-  gen_x<<<148 * 8, 256>>>(ncols, x);
+  gen_cols<<<g_sms * 8, 256>>>(nnz, ncols, cols);
+  gen_x<<<g_sms * 8, 256>>>(ncols, x);
   CK(cudaDeviceSynchronize());
 
   // ---- LSU paths
-  run("lsu   ld.global.nc.f64  unroll 1 (4 in flight)", nnz, iters, 0, [&] { k_lsu<1, false><<<148 * 8, 256>>>(nnz, cols, x, d_out); });
+  run("lsu   ld.global.nc.f64  unroll 1 (4 in flight)", nnz, iters, 0, [&] { k_lsu<1, false><<<g_sms * 8, 256>>>(nnz, cols, x, d_out); });
   // SM clock right after a loaded kernel
   k_clock<<<1, 1>>>(d_mhz); CK(cudaDeviceSynchronize());
   CK(cudaMemcpy(&g_mhz, d_mhz, 8, cudaMemcpyDeviceToHost));
-  printf("SM clock measured in-kernel: %.0f MHz (1 gather/clk/SM = %.1f Ggather/s)\n", g_mhz, g_mhz * 148 / 1e3);
-  run("lsu   ld.global.nc.f64  unroll 1", nnz, iters, ref_sum, [&] { k_lsu<1, false><<<148 * 8, 256>>>(nnz, cols, x, d_out); });
-  run("lsu   ld.global.nc.f64  unroll 2 (8 in flight)", nnz, iters, ref_sum, [&] { k_lsu<2, false><<<148 * 8, 256>>>(nnz, cols, x, d_out); });
-  run("lsu   ld.global.nc.f64  unroll 4 (16 in flight)", nnz, iters, ref_sum, [&] { k_lsu<4, false><<<148 * 8, 256>>>(nnz, cols, x, d_out); });
-  run("lsu   unroll 2, 4 CTAs/SM", nnz, iters, ref_sum, [&] { k_lsu<2, false><<<148 * 4, 256>>>(nnz, cols, x, d_out); });
-  run("lsu16 ld.global.nc.v2.f64 unroll 2", nnz, iters, ref_sum, [&] { k_lsu<2, true><<<148 * 8, 256>>>(nnz, cols, x, d_out); });
+  printf("SM clock measured in-kernel: %.0f MHz (1 gather/clk/SM = %.1f Ggather/s)\n", g_mhz, g_mhz * g_sms / 1e3);
+  run("lsu   ld.global.nc.f64  unroll 1", nnz, iters, ref_sum, [&] { k_lsu<1, false><<<g_sms * 8, 256>>>(nnz, cols, x, d_out); });
+  run("lsu   ld.global.nc.f64  unroll 2 (8 in flight)", nnz, iters, ref_sum, [&] { k_lsu<2, false><<<g_sms * 8, 256>>>(nnz, cols, x, d_out); });
+  run("lsu   ld.global.nc.f64  unroll 4 (16 in flight)", nnz, iters, ref_sum, [&] { k_lsu<4, false><<<g_sms * 8, 256>>>(nnz, cols, x, d_out); });
+  run("lsu   unroll 2, 4 CTAs/SM", nnz, iters, ref_sum, [&] { k_lsu<2, false><<<g_sms * 4, 256>>>(nnz, cols, x, d_out); });
+  run("lsu16 ld.global.nc.v2.f64 unroll 2", nnz, iters, ref_sum, [&] { k_lsu<2, true><<<g_sms * 8, 256>>>(nnz, cols, x, d_out); });
 
   // ---- cp.async (LDGSTS) gathers into shared memory: DEPTH x 4 gathers per thread in flight, no registers held.
   // `smem KB/SM` is what the resident CTAs allocate: the driver sizes the L1 with what is left of 256 KB, and the
@@ -465,7 +435,7 @@ int main(int argc, char** argv) {
       CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
       CK(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
       char name[128]; snprintf(name, sizeof name, "ldgsts %s, %2d in flight/thread, CTAs/SM=%d, smem %3zu KB/SM", what, depth * 4, ctas, sm * ctas / 1024);
-      run(name, nnz, iters, ref_sum, [&] { kern<<<148 * ctas, 256, sm>>>(nnz, cols, x, d_out); });
+      run(name, nnz, iters, ref_sum, [&] { kern<<<g_sms * ctas, 256, sm>>>(nnz, cols, x, d_out); });
     };
     for (int ctas : {2, 4}) {
       for (size_t pad : {(size_t)0, (size_t)32}) {
@@ -482,80 +452,24 @@ int main(int argc, char** argv) {
   if (getenv("GATHER_FLAVOURS")) {
     const char* fl[3] = {"nc", "nc.L1::no_allocate", "cg"};
     for (int ctas : {4, 8}) {
-      run((std::string("lsu ") + fl[0] + "  4 in flight, CTAs/SM=" + std::to_string(ctas)).c_str(), nnz, iters, ref_sum, [&] { k_lsu_mode<0, 4><<<148 * ctas, 256>>>(nnz, cols, x, d_out); });
-      run((std::string("lsu ") + fl[1] + "  4 in flight, CTAs/SM=" + std::to_string(ctas)).c_str(), nnz, iters, ref_sum, [&] { k_lsu_mode<1, 4><<<148 * ctas, 256>>>(nnz, cols, x, d_out); });
-      run((std::string("lsu ") + fl[2] + "  4 in flight, CTAs/SM=" + std::to_string(ctas)).c_str(), nnz, iters, ref_sum, [&] { k_lsu_mode<2, 4><<<148 * ctas, 256>>>(nnz, cols, x, d_out); });
-      run((std::string("lsu ") + fl[0] + " 16 in flight, CTAs/SM=" + std::to_string(ctas)).c_str(), nnz, iters, ref_sum, [&] { k_lsu_mode<0, 16><<<148 * ctas, 256>>>(nnz, cols, x, d_out); });
-      run((std::string("lsu ") + fl[1] + " 16 in flight, CTAs/SM=" + std::to_string(ctas)).c_str(), nnz, iters, ref_sum, [&] { k_lsu_mode<1, 16><<<148 * ctas, 256>>>(nnz, cols, x, d_out); });
-      run((std::string("lsu ") + fl[2] + " 16 in flight, CTAs/SM=" + std::to_string(ctas)).c_str(), nnz, iters, ref_sum, [&] { k_lsu_mode<2, 16><<<148 * ctas, 256>>>(nnz, cols, x, d_out); });
+      run((std::string("lsu ") + fl[0] + "  4 in flight, CTAs/SM=" + std::to_string(ctas)).c_str(), nnz, iters, ref_sum, [&] { k_lsu_mode<0, 4><<<g_sms * ctas, 256>>>(nnz, cols, x, d_out); });
+      run((std::string("lsu ") + fl[1] + "  4 in flight, CTAs/SM=" + std::to_string(ctas)).c_str(), nnz, iters, ref_sum, [&] { k_lsu_mode<1, 4><<<g_sms * ctas, 256>>>(nnz, cols, x, d_out); });
+      run((std::string("lsu ") + fl[2] + "  4 in flight, CTAs/SM=" + std::to_string(ctas)).c_str(), nnz, iters, ref_sum, [&] { k_lsu_mode<2, 4><<<g_sms * ctas, 256>>>(nnz, cols, x, d_out); });
+      run((std::string("lsu ") + fl[0] + " 16 in flight, CTAs/SM=" + std::to_string(ctas)).c_str(), nnz, iters, ref_sum, [&] { k_lsu_mode<0, 16><<<g_sms * ctas, 256>>>(nnz, cols, x, d_out); });
+      run((std::string("lsu ") + fl[1] + " 16 in flight, CTAs/SM=" + std::to_string(ctas)).c_str(), nnz, iters, ref_sum, [&] { k_lsu_mode<1, 16><<<g_sms * ctas, 256>>>(nnz, cols, x, d_out); });
+      run((std::string("lsu ") + fl[2] + " 16 in flight, CTAs/SM=" + std::to_string(ctas)).c_str(), nnz, iters, ref_sum, [&] { k_lsu_mode<2, 16><<<g_sms * ctas, 256>>>(nnz, cols, x, d_out); });
     }
     return 0;
   }
 
-  // ---- TMA gather4: tensor map over x as [ncols/2][2] fp64
-  EncodeTiled_t encode = nullptr;
-  cudaDriverEntryPointQueryResult qres;
-  CK(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", (void**)&encode, cudaEnableDefault, &qres));
-  if (!encode || qres != cudaDriverEntryPointSuccess) { printf("cuTensorMapEncodeTiled unavailable\n"); return 1; }
-  CUtensorMap tm_ok; bool have_tm = false;
-  for (int boxrows = 1; boxrows <= 4 && !have_tm; boxrows += 3) {
-    CUtensorMap tm;
-    cuuint64_t gdim[2] = {2, (cuuint64_t)(ncols / 2)};
-    cuuint64_t gstr[1] = {16};
-    cuuint32_t box[2] = {2, (cuuint32_t)boxrows};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult r = encode(&tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT64, 2, x, gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                        CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { printf("gather4 probe: encode with box rows=%d failed (%d)\n", boxrows, (int)r); continue; }
-    int rows[4] = {5, 1000, 77, (int)(ncols / 2 - 1)};
-    k_g4_probe<<<1, 1>>>(tm, rows[0], rows[1], rows[2], rows[3], d_out, d_err);
-    cudaError_t e = cudaDeviceSynchronize();
-    if (e != cudaSuccess) { printf("gather4 probe (box rows=%d): kernel failed: %s\n", boxrows, cudaGetErrorString(e)); return 1; }
-    double h[17]; CK(cudaMemcpy(h, d_out, sizeof h, cudaMemcpyDeviceToHost));
-    std::vector<double> hx(8);
-    bool good = h[16] == 1.0;
-    for (int k = 0; k < 4 && good; ++k) {
-      double want[2]; CK(cudaMemcpy(want, x + (int64_t)rows[k] * 2, 16, cudaMemcpyDeviceToHost));
-      good = good && h[2 * k] == want[0] && h[2 * k + 1] == want[1];
-    }
-    printf("gather4 probe, tensor-map box {2,%d}: completed=%d, rows land as 4 consecutive 16-byte chunks: %s\n", boxrows, (int)h[16],
-           good ? "YES" : "no");
-    CK(cudaMemset(d_err, 0, 4));
-    if (good) { tm_ok = tm; have_tm = true; }
-  }
-  if (have_tm) {
-    // pure TMA rate (the LSU only reads the results out of shared memory), then without the read-out
-    run_tma<2, 512, 512, 4, false>("g4    ", tm_ok, nnz, cols, x, iters, 1, 1, ref_sum);
-    run_tma<2, 512, 512, 4, false>("g4    ", tm_ok, nnz, cols, x, iters, 2, 1, ref_sum);
-    run_tma<2, 512, 512, 4, false>("g4    ", tm_ok, nnz, cols, x, iters, 4, 1, ref_sum);
-    run_tma<2, 256, 256, 4, false>("g4    ", tm_ok, nnz, cols, x, iters, 8, 1, ref_sum);
-    run_tma<2, 512, 512, 4, false>("g4    ", tm_ok, nnz, cols, x, iters, 4, 0, ref_sum);
-  }
-  {
-    CUtensorMap dummy; memset(&dummy, 0, sizeof dummy);
-    run_tma<2, 512, 512, 4, true>("bulk16", dummy, nnz, cols, x, iters, 1, 1, ref_sum);
-    run_tma<2, 512, 512, 4, true>("bulk16", dummy, nnz, cols, x, iters, 4, 1, ref_sum);
-    run_tma<2, 256, 256, 4, true>("bulk16", dummy, nnz, cols, x, iters, 8, 1, ref_sum);
-    run_tma<2, 512, 512, 4, true>("bulk16", dummy, nnz, cols, x, iters, 4, 0, ref_sum);
-  }
-  if (have_tm) {
-    // both paths at once: 8 LSU warps + 1 TMA producer warp per CTA
-    run_tma<8, 2048, 0, 2, false>("mix   ", tm_ok, nnz, cols, x, iters, 2, 1, ref_sum);
-    run_tma<8, 2048, 0, 2, false>("mix   ", tm_ok, nnz, cols, x, iters, 3, 1, ref_sum);
-    run_tma<8, 2048, 0, 2, false>("mix   ", tm_ok, nnz, cols, x, iters, 4, 1, ref_sum);
-    run_tma<8, 2048, 128, 2, false>("mix   ", tm_ok, nnz, cols, x, iters, 2, 1, ref_sum);
-    run_tma<8, 2048, 256, 2, false>("mix   ", tm_ok, nnz, cols, x, iters, 2, 1, ref_sum);
-    run_tma<8, 2048, 512, 2, false>("mix   ", tm_ok, nnz, cols, x, iters, 2, 1, ref_sum);
-    run_tma<8, 2048, 768, 2, false>("mix   ", tm_ok, nnz, cols, x, iters, 2, 1, ref_sum);
-    run_tma<8, 2048, 1024, 2, false>("mix   ", tm_ok, nnz, cols, x, iters, 2, 1, ref_sum);
-    run_tma<8, 2048, 256, 2, false>("mix   ", tm_ok, nnz, cols, x, iters, 3, 1, ref_sum);
-    run_tma<8, 2048, 512, 2, false>("mix   ", tm_ok, nnz, cols, x, iters, 3, 1, ref_sum);
-    run_tma<8, 2048, 256, 2, false>("mix   ", tm_ok, nnz, cols, x, iters, 4, 1, ref_sum);
-    run_tma<8, 2048, 512, 2, false>("mix   ", tm_ok, nnz, cols, x, iters, 4, 1, ref_sum);
-    CUtensorMap dummy; memset(&dummy, 0, sizeof dummy);
-    run_tma<8, 2048, 256, 2, true>("mixb16", dummy, nnz, cols, x, iters, 2, 1, ref_sum);
-    run_tma<8, 2048, 512, 2, true>("mixb16", dummy, nnz, cols, x, iters, 2, 1, ref_sum);
-  }
+  // ---- bulk16: producer warp stages the gathers with 16-byte cp.async.bulk copies
+  run_tma<2, 512, 512, 4>("bulk16", nnz, cols, x, iters, 1, 1, ref_sum);
+  run_tma<2, 512, 512, 4>("bulk16", nnz, cols, x, iters, 4, 1, ref_sum);
+  run_tma<2, 256, 256, 4>("bulk16", nnz, cols, x, iters, 8, 1, ref_sum);
+  run_tma<2, 512, 512, 4>("bulk16", nnz, cols, x, iters, 4, 0, ref_sum);
+  // both paths at once: 8 LSU warps + 1 bulk-copy producer warp per CTA
+  run_tma<8, 2048, 256, 2>("mixb16", nnz, cols, x, iters, 2, 1, ref_sum);
+  run_tma<8, 2048, 512, 2>("mixb16", nnz, cols, x, iters, 2, 1, ref_sum);
 
   // ---- DSMEM: x slice in the shared memory of a cluster
   {
@@ -587,7 +501,7 @@ int main(int argc, char** argv) {
       CK(cudaDeviceSynchronize());
       double got, want; CK(cudaMemcpy(&got, d_out, 8, cudaMemcpyDeviceToHost));
       CK(cudaMemset(d_out, 0, 8));
-      k_mod_ref<<<148 * 8, 256>>>(per_cluster * nclusters, cols, x, (uint32_t)(cs * SLICE), d_out);
+      k_mod_ref<<<g_sms * 8, 256>>>(per_cluster * nclusters, cols, x, (uint32_t)(cs * SLICE), d_out);
       CK(cudaDeviceSynchronize());
       CK(cudaMemcpy(&want, d_out, 8, cudaMemcpyDeviceToHost));
       t.start();

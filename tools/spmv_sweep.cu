@@ -228,8 +228,8 @@ int main(int argc, char** argv) {
     gen_poisson<int32_t><<<(unsigned)((n + 255) / 256), 256>>>(gridN, c32, vals, indptr);
     gen_poisson<int64_t><<<(unsigned)((n + 255) / 256), 256>>>(gridN, c64, vals, indptr);
   } else {
-    gen_random<int32_t><<<148 * 16, 256>>>(n, m, k, c32, vals, indptr);
-    gen_random<int64_t><<<148 * 16, 256>>>(n, m, k, c64, vals, indptr);
+    gen_random<int32_t><<<prop.multiProcessorCount * 16, 256>>>(n, m, k, c32, vals, indptr);
+    gen_random<int64_t><<<prop.multiProcessorCount * 16, 256>>>(n, m, k, c64, vals, indptr);
   }
   fill_x<<<(unsigned)((m + 255) / 256), 256>>>(m, x);
   CK(cudaDeviceSynchronize());
@@ -245,14 +245,14 @@ int main(int argc, char** argv) {
   // ceilings
   {
     Timer t;
-    for (int w = 0; w < 2; ++w) stream_kernel<int32_t><<<148 * 32, 256>>>(nnz, c32, vals, sink);
+    for (int w = 0; w < 2; ++w) stream_kernel<int32_t><<<prop.multiProcessorCount * 32, 256>>>(nnz, c32, vals, sink);
     t.start();
-    for (int i = 0; i < iters; ++i) stream_kernel<int32_t><<<148 * 32, 256>>>(nnz, c32, vals, sink);
+    for (int i = 0; i < iters; ++i) stream_kernel<int32_t><<<prop.multiProcessorCount * 32, 256>>>(nnz, c32, vals, sink);
     float ms = t.stop() / iters;
     printf("ceiling stream (col32+val)            : %8.3f ms  %7.1f GB/s\n", ms, nnz * 12.0 / ms / 1e6);
-    for (int w = 0; w < 2; ++w) gather_kernel<1><<<148 * 32, 256>>>(nnz, c32, x, sink);
+    for (int w = 0; w < 2; ++w) gather_kernel<1><<<prop.multiProcessorCount * 32, 256>>>(nnz, c32, x, sink);
     t.start();
-    for (int i = 0; i < iters; ++i) gather_kernel<1><<<148 * 32, 256>>>(nnz, c32, x, sink);
+    for (int i = 0; i < iters; ++i) gather_kernel<1><<<prop.multiProcessorCount * 32, 256>>>(nnz, c32, x, sink);
     ms = t.stop() / iters;
     printf("ceiling gather (col32 + x[col])       : %8.3f ms  %7.1f Ggather/s\n", ms, nnz / ms / 1e6);
     CK(cudaDeviceSynchronize());
